@@ -228,7 +228,12 @@ int  mxd_host_unregister(mxd_ctx*, void* p);
  * Inputs and outputs are device pointers on device `dev` (index into the context's device list);
  * work is enqueued on `stream` (a cudaStream_t; NULL = the legacy default stream) and the call
  * returns without synchronising.  Used by bench.py (kernel-only timing) and by callers that
- * already hold blobs in HBM. */
+ * already hold blobs in HBM.
+ * Alignment: message bytes (d_data, d_piece, span pointers) may start at any address.  Digest
+ * outputs (d_out, d_chunk_digests, d_root) and the chunk-digest input of mxd_dev_tree_finish must
+ * be 16-byte aligned, d_spans 8-byte aligned, and mxd_dev_gen_fill's d_dst, offset and n multiples
+ * of 8.  A data pointer may be NULL only when its length is 0.  A call that breaks one of these
+ * rules returns MXD_ERR_INVALID and enqueues nothing. */
 int mxd_dev_sha256_segments(mxd_ctx*, int dev, const void* d_data, uint64_t nbytes, uint64_t seg,
                             void* d_out /*ceil(nbytes/seg)*32*/, void* stream);
 int mxd_dev_sha256_batch(mxd_ctx*, int dev, const mxd_span* d_spans /*device array*/, uint64_t n, void* d_out, void* stream);

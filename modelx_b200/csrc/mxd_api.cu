@@ -846,15 +846,19 @@ int mxd_tree_shape(uint64_t size, const mxd_tree_params* tp, uint64_t* counts, i
 }
 
 #define DEV_ARGS_OK(h, dev) (handle_ok(h) && (dev) >= 0 && (dev) < (int)(h)->core->devs.size())
+// The kernels store digests as uint4 and k_tree_top reads digests as 32-bit words; spans are read as 8-byte fields.
+static bool aligned_to(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 int mxd_dev_sha256_segments(mxd_ctx* h, int dev, const void* d_data, uint64_t nbytes, uint64_t seg, void* d_out, void* stream) {
-    if (!DEV_ARGS_OK(h, dev) || seg == 0 || !d_out) return fail(MXD_ERR_INVALID, "dev_sha256_segments: bad arguments");
+    if (!DEV_ARGS_OK(h, dev) || seg == 0 || !d_out || !aligned_to(d_out, 16) || (nbytes && !d_data))
+        return fail(MXD_ERR_INVALID, "dev_sha256_segments: bad arguments");
     DeviceGuard guard(h->core->devs[dev]->ordinal);
     return enqueue_segments(h->core, static_cast<const uint8_t*>(d_data), nbytes, seg, static_cast<uint8_t*>(d_out), (cudaStream_t)stream);
 }
 
 int mxd_dev_sha256_batch(mxd_ctx* h, int dev, const mxd_span* d_spans, uint64_t n, void* d_out, void* stream) {
-    if (!DEV_ARGS_OK(h, dev) || (n && (!d_spans || !d_out))) return fail(MXD_ERR_INVALID, "dev_sha256_batch: bad arguments");
+    if (!DEV_ARGS_OK(h, dev) || (n && (!d_spans || !d_out)) || !aligned_to(d_spans, 8) || !aligned_to(d_out, 16))
+        return fail(MXD_ERR_INVALID, "dev_sha256_batch: bad arguments");
     if (n == 0) return MXD_OK;
     DeviceGuard guard(h->core->devs[dev]->ordinal);
     mxd::MsgJob j{};
@@ -867,7 +871,7 @@ int mxd_dev_sha256_batch(mxd_ctx* h, int dev, const mxd_span* d_spans, uint64_t 
 int mxd_dev_tree_chunks(mxd_ctx* h, int dev, const void* d_piece, uint64_t nbytes, const mxd_tree_params* tp,
                         void* d_chunk_digests, void* stream) {
     Tree t;
-    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_chunk_digests)
+    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_chunk_digests || !aligned_to(d_chunk_digests, 16) || (nbytes && !d_piece))
         return fail(MXD_ERR_INVALID, "dev_tree_chunks: bad arguments");
     DeviceGuard guard(h->core->devs[dev]->ordinal);
     return enqueue_tree_chunks(h->core, t, static_cast<const uint8_t*>(d_piece), nbytes, static_cast<uint8_t*>(d_chunk_digests),
@@ -877,7 +881,8 @@ int mxd_dev_tree_chunks(mxd_ctx* h, int dev, const void* d_piece, uint64_t nbyte
 int mxd_dev_tree_finish(mxd_ctx* h, int dev, const void* d_chunk_digests, uint64_t nchunks, uint64_t size,
                         const mxd_tree_params* tp, void* d_root, void* stream) {
     Tree t;
-    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_chunk_digests || !d_root || nchunks == 0)
+    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_chunk_digests || !d_root || nchunks == 0 ||
+        !aligned_to(d_chunk_digests, 16) || !aligned_to(d_root, 16))
         return fail(MXD_ERR_INVALID, "dev_tree_finish: bad arguments");
     DeviceGuard guard(h->core->devs[dev]->ordinal);
     return enqueue_tree_finish(h->core, t, static_cast<const uint8_t*>(d_chunk_digests), nchunks, size,
@@ -887,7 +892,8 @@ int mxd_dev_tree_finish(mxd_ctx* h, int dev, const void* d_chunk_digests, uint64
 int mxd_dev_tree_digest(mxd_ctx* h, int dev, const void* d_data, uint64_t size, const mxd_tree_params* tp,
                         void* d_chunk_digests, void* d_root, void* stream) {
     Tree t;
-    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_root)
+    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || !d_root || !aligned_to(d_root, 16) || !aligned_to(d_chunk_digests, 16) ||
+        (size && !d_data))
         return fail(MXD_ERR_INVALID, "dev_tree_digest: bad arguments");
     Core* c = h->core;
     DeviceGuard guard(c->devs[dev]->ordinal);
@@ -912,7 +918,8 @@ int mxd_dev_compare(mxd_ctx* h, int dev, const void* d_got, const void* d_want, 
 }
 
 int mxd_dev_gen_fill(mxd_ctx* h, int dev, void* d_dst, uint64_t offset, uint64_t n, uint64_t seed, void* stream) {
-    if (!DEV_ARGS_OK(h, dev) || (n && !d_dst)) return fail(MXD_ERR_INVALID, "dev_gen_fill: bad arguments");
+    if (!DEV_ARGS_OK(h, dev) || (n && !d_dst) || !aligned_to(d_dst, 8) || ((offset | n) & 7u))
+        return fail(MXD_ERR_INVALID, "dev_gen_fill: bad arguments");
     DeviceGuard guard(h->core->devs[dev]->ordinal);
     MXD_CUDA(mxd::launch_gen_fill(d_dst, offset, n, seed, (cudaStream_t)stream));
     if (n) h->core->launches++;

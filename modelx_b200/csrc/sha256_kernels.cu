@@ -201,6 +201,9 @@ __global__ void __launch_bounds__(THREADS, MINB) k_sha256_lanes(const MsgJob j) 
 constexpr int kCoopStages = 2;                     // blocks the producer may run ahead
 constexpr int kFull0 = 1, kEmpty0 = 1 + kCoopStages;   // named barrier ids (0 is __syncthreads)
 
+__device__ __forceinline__ uint32_t mad_lo(uint32_t a, uint32_t b, uint32_t c) {        // a*b+c on the FMA pipe
+    uint32_t d; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d;
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(nthreads) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" :: "r"(id), "r"(nthreads) : "memory"); }
 
@@ -357,7 +360,7 @@ __global__ void __launch_bounds__(64) k_sha256_chains_coop(const MsgJob j) {
                         const uint32_t x = add_fma(wkh, d, one);                 // no dependence on e: off the critical path
                         const uint32_t y = add_fma(x, ch(e, f, gg), one);
                         const uint32_t enew = add_fma(y, big_sigma1(e), one);
-                        const uint32_t t1 = add_fma(d, minus_one, enew);          // T1 = e' - d
+                        const uint32_t t1 = mad_lo(d, minus_one, enew);           // T1 = e' - d
                         const uint32_t z = add_fma(t1, maj(a, bb, c), one);
                         hh = add_fma(z, big_sigma0(a), one);
                         d = enew;
@@ -429,9 +432,6 @@ constexpr int kPairFull0 = 1, kPairEmpty0 = 3;     // named barriers per PAIR of
 template <int LUT>
 __device__ __forceinline__ uint32_t lop3(uint32_t a, uint32_t b, uint32_t c) {
     uint32_t d; asm("lop3.b32 %0, %1, %2, %3, %4;" : "=r"(d) : "r"(a), "r"(b), "r"(c), "n"(LUT)); return d;
-}
-__device__ __forceinline__ uint32_t mad_lo(uint32_t a, uint32_t b, uint32_t c) {        // a*b+c on the FMA pipe
-    uint32_t d; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d;
 }
 
 // Producer warp of the pair kernel.  Only 16 chains per CTA, so the warp's two halves work on two CONSECUTIVE blocks of

@@ -243,6 +243,21 @@ int mxd_dev_tree_finish(mxd_ctx*, int dev, const void* d_chunk_digests, uint64_t
                         const mxd_tree_params* tp, void* d_root /*32*/, void* stream);
 int mxd_dev_tree_digest(mxd_ctx*, int dev, const void* d_data, uint64_t size, const mxd_tree_params* tp,
                         void* d_chunk_digests /*may be NULL*/, void* d_root /*32*/, void* stream);
+/* The tree digest of the concatenation extents[0] || extents[1] || ... || extents[n-1], each a device span on device
+ * `dev` -- e.g. a safetensors header followed by the tensors it describes, without gathering them into one buffer.
+ * Results are bit-identical to mxd_dev_tree_digest on one buffer holding the same bytes.  `extents` is a HOST array;
+ * the library keeps no pointer to it after the call returns.  Enqueued on `stream`, asynchronous like the calls above.
+ *   - Extents may start at any byte address and have any length, including 0.  The same pointer may appear more than
+ *     once and extents may overlap: they are only read.
+ *   - n == 0, or only empty extents, is the empty blob.
+ *   - d_root, and d_chunk_digests when not NULL (nchunks * 32 bytes), must be 16-byte aligned.
+ *   - Returns MXD_ERR_INVALID and enqueues nothing when the handle or `dev` is bad, n > 0 and extents == NULL, an extent
+ *     with a nonzero length has a NULL pointer, the total length overflows uint64_t, the tree parameters are invalid,
+ *     or an output is NULL where required or misaligned.  Extent pointers are not inspected otherwise.
+ *   - Device scratch: the leaf digests (32 bytes per leaf) and a 24-byte table entry per non-empty extent, allocated
+ *     and freed in stream order. */
+int mxd_dev_tree_digest_extents(mxd_ctx*, int dev, const mxd_span* extents, uint64_t n, const mxd_tree_params* tp,
+                                void* d_chunk_digests /*nchunks*32, may be NULL*/, void* d_root /*32*/, void* stream);
 int mxd_dev_compare(mxd_ctx*, int dev, const void* d_got, const void* d_want, uint64_t n, void* d_ok /*n bytes*/, void* stream);
 /* deterministic synthetic blob (benchmarks/tests): LE64 word j = splitmix64(seed, j); offset, n multiples of 8 */
 int mxd_dev_gen_fill(mxd_ctx*, int dev, void* d_dst, uint64_t offset, uint64_t n, uint64_t seed, void* stream);

@@ -110,6 +110,7 @@ PROTOTYPES = {
     "mxd_dev_tree_chunks": (C.c_int, [vp, C.c_int, vp, C.c_uint64, C.POINTER(TreeParams), vp, vp]),
     "mxd_dev_tree_finish": (C.c_int, [vp, C.c_int, vp, C.c_uint64, C.c_uint64, C.POINTER(TreeParams), vp, vp]),
     "mxd_dev_tree_digest": (C.c_int, [vp, C.c_int, vp, C.c_uint64, C.POINTER(TreeParams), vp, vp, vp]),
+    "mxd_dev_tree_digest_extents": (C.c_int, [vp, C.c_int, C.POINTER(Span), C.c_uint64, C.POINTER(TreeParams), vp, vp, vp]),
     "mxd_dev_compare": (C.c_int, [vp, C.c_int, vp, vp, C.c_uint64, vp, vp]),
     "mxd_dev_gen_fill": (C.c_int, [vp, C.c_int, vp, C.c_uint64, C.c_uint64, C.c_uint64, vp]),
 }

@@ -70,6 +70,23 @@ uint64_t leaf_sched_bytes(uint64_t n0);
 bool leaf_kernel_selected();
 // How many tree levels launch_tree_leaves will fuse for this fanout when asked for at most `want` levels.
 uint32_t leaf_fusable_levels(uint32_t fanout, uint32_t want);
+// One piece of a blob that is scattered over device buffers: `len` (> 0) bytes at `ptr` (any alignment), which are bytes
+// [start, start + len) of the concatenation.
+struct DevExtent { const void* ptr; uint64_t len; uint64_t start; };
+
+// The leaf level of a tree digest over a concatenation of extents: leaf i = SHA-256 of bytes [i*leaf, min((i+1)*leaf,
+// size)) of the concatenation (one empty leaf when size == 0), written to out + 32 i.
+struct ExtentLeafJob {
+    const DevExtent* ext;    // device table of m extents in concatenation order (may be NULL when m == 0)
+    uint64_t m;
+    uint64_t size;           // sum of the extent lengths
+    uint64_t leaf;           // bytes per leaf, multiple of 64
+    uint64_t n0;             // max(1, ceil(size / leaf))
+    uint8_t* out;            // n0 * 32 bytes, 16-byte aligned
+    uint32_t one;
+};
+cudaError_t launch_tree_leaves_extents(const ExtentLeafJob& job, cudaStream_t stream);
+
 // All levels above a digest list (n >= 1 digests of 32 bytes, groups of `fanout`) and the root message, one launch:
 // root = SHA256("modelx.tree.v1\0\0" || LE64(size) || LE64(leaf) || LE32(fanout) || LE32(0) || top[32]).
 // scratch: device memory of tree_top_scratch_bytes(n, fanout) bytes.
@@ -81,7 +98,8 @@ cudaError_t launch_compare(const uint8_t* got, const uint8_t* want, uint64_t n, 
 // bytes [offset, offset+n) of the splitmix64 counter stream (offset and n multiples of 8, dst 8-byte aligned)
 cudaError_t launch_gen_fill(void* dst, uint64_t offset, uint64_t n, uint64_t seed, cudaStream_t stream);
 int sha256_kernel_regs();
-// kernels this library has launched in this process (every <<<>>> of sha256_kernels.cu counts one)
+// kernels this library has launched in this process (every <<<>>> of the library counts one)
 uint64_t kernel_launch_count();
+void count_kernel_launch();
 
 }  // namespace mxd

@@ -541,6 +541,29 @@ bool handle_ok(const mxd_ctx* h) { return h != nullptr && h->core != nullptr; }
 }  // namespace
 }  // namespace mxdi
 
+#ifdef MXD_MOCK_CUDA
+namespace mxd {
+// Only in the CPU test double (tests/mock), which compiles the host sources of this library with its own kernel
+// launchers and has none for k_tree_leaves_extents: there the leaf level is the concatenation gathered into one
+// buffer and hashed as uniform leaf-sized segments through launch_sha256, so the host logic of
+// mxd_dev_tree_digest_extents runs unchanged.  The CUDA build never compiles this.
+cudaError_t launch_tree_leaves_extents(const ExtentLeafJob& j, cudaStream_t st) {
+    if (j.n0 == 0 || (j.size != 0 && (j.m == 0 || j.ext == nullptr)) || j.out == nullptr) return cudaErrorInvalidValue;
+    uint8_t* cat = nullptr;
+    cudaError_t e = cudaMallocAsync(&cat, j.size ? j.size : 1, st);
+    for (uint64_t i = 0; e == cudaSuccess && i < j.m; ++i)
+        e = cudaMemcpyAsync(cat + j.ext[i].start, j.ext[i].ptr, j.ext[i].len, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) {
+        MsgJob m{};
+        m.base = cat; m.nbytes = j.size; m.seg = j.leaf; m.nmsg = j.n0; m.out = j.out; m.finalize = 1; m.one = j.one;
+        e = launch_sha256(m, st);
+    }
+    if (cat) cudaFreeAsync(cat, st);
+    return e;
+}
+}  // namespace mxd
+#endif
+
 using namespace mxdi;
 
 // =================================================================================================
@@ -904,6 +927,58 @@ int mxd_dev_tree_digest(mxd_ctx* h, int dev, const void* d_data, uint64_t size, 
     if (!chunks) { MXD_CUDA(cudaMallocAsync(&owned, nchunks * 32, st)); chunks = owned; }
     int rc = enqueue_tree_chunks(c, t, static_cast<const uint8_t*>(d_data), size, chunks, st);
     if (rc == MXD_OK) rc = enqueue_tree_finish(c, t, chunks, nchunks, size, static_cast<uint8_t*>(d_root), st);
+    if (owned) cudaFreeAsync(owned, st);
+    return rc;
+}
+
+int mxd_dev_tree_digest_extents(mxd_ctx* h, int dev, const mxd_span* extents, uint64_t n, const mxd_tree_params* tp,
+                                void* d_chunk_digests, void* d_root, void* stream) {
+    Tree t;
+    if (!DEV_ARGS_OK(h, dev) || !tree_resolve(tp, &t) || (n && !extents) || !d_root || !aligned_to(d_root, 16) ||
+        !aligned_to(d_chunk_digests, 16))
+        return fail(MXD_ERR_INVALID, "dev_tree_digest_extents: bad arguments");
+    // the device table: non-empty extents in order, each with its offset in the concatenation
+    std::vector<mxd::DevExtent> table;
+    uint64_t size = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        if (extents[i].len == 0) continue;
+        if (!extents[i].ptr) return fail(MXD_ERR_INVALID, "dev_tree_digest_extents: extent " + std::to_string(i) + " is NULL with a nonzero length");
+        if (extents[i].len > ~0ull - size) return fail(MXD_ERR_INVALID, "dev_tree_digest_extents: total length overflows 64 bits");
+        table.push_back({extents[i].ptr, extents[i].len, size});
+        size += extents[i].len;
+    }
+    Core* c = h->core;
+    DeviceGuard guard(c->devs[dev]->ordinal);
+    cudaStream_t st = (cudaStream_t)stream;
+    const uint64_t nchunks = size ? (size + t.chunk - 1) / t.chunk : 1;
+    const uint64_t n0 = size ? (size + t.leaf - 1) / t.leaf : 1;
+    uint8_t* chunks = static_cast<uint8_t*>(d_chunk_digests);
+    uint8_t* owned = nullptr;
+    mxd::DevExtent* d_table = nullptr;
+    uint8_t* ws = nullptr;
+    if (!chunks) { MXD_CUDA(cudaMallocAsync(&owned, nchunks * 32, st)); chunks = owned; }
+    int rc = MXD_OK;
+    cudaError_t e = cudaMallocAsync(&ws, n0 * 32, st);
+    if (e == cudaSuccess && !table.empty()) {
+        e = cudaMallocAsync(&d_table, table.size() * sizeof(mxd::DevExtent), st);
+        // From pageable memory, cudaMemcpyAsync returns only after the source has been staged, so `table` (and the
+        // caller's array) may go away when this call returns.
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(mxd::DevExtent), cudaMemcpyHostToDevice, st);
+    }
+    if (e != cudaSuccess) rc = fail(MXD_ERR_CUDA, std::string("dev_tree_digest_extents: ") + cudaGetErrorString(e));
+    if (rc == MXD_OK) {
+        ProfScope prof(c, size, st);
+        mxd::ExtentLeafJob j{};
+        j.ext = d_table; j.m = table.size(); j.size = size; j.leaf = t.leaf; j.n0 = n0; j.out = ws; j.one = 1;
+        e = mxd::launch_tree_leaves_extents(j, st);
+        if (e != cudaSuccess) rc = fail(MXD_ERR_CUDA, std::string("launch_tree_leaves_extents: ") + cudaGetErrorString(e));
+        else { c->launches++; c->bytes_hashed += size; }
+    }
+    if (rc == MXD_OK) rc = enqueue_levels_to_chunks(c, t, 0, ws, n0, chunks, st);
+    if (rc == MXD_OK) rc = enqueue_tree_finish(c, t, chunks, nchunks, size, static_cast<uint8_t*>(d_root), st);
+    if (d_table) cudaFreeAsync(d_table, st);
+    if (ws) cudaFreeAsync(ws, st);
     if (owned) cudaFreeAsync(owned, st);
     return rc;
 }

@@ -111,4 +111,27 @@ __device__ __forceinline__ void sha256_compress(uint32_t (&h)[8], uint32_t (&w)[
     for (int i = 0; i < 8; ++i) h[i] = add_fma(h[i], s[i], one);
 }
 
+// ---- block loads and digest stores shared by the kernels -----------------------------------------
+__device__ __forceinline__ uint4 ldg128(const uint4* p) {
+    uint4 v;
+    asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+    return v;
+}
+
+__device__ __forceinline__ void unpack_block(const uint4& v0, const uint4& v1, const uint4& v2, const uint4& v3,
+                                             uint32_t (&w)[16]) {
+    w[0] = bswap32(v0.x);  w[1] = bswap32(v0.y);  w[2] = bswap32(v0.z);  w[3] = bswap32(v0.w);
+    w[4] = bswap32(v1.x);  w[5] = bswap32(v1.y);  w[6] = bswap32(v1.z);  w[7] = bswap32(v1.w);
+    w[8] = bswap32(v2.x);  w[9] = bswap32(v2.y);  w[10] = bswap32(v2.z); w[11] = bswap32(v2.w);
+    w[12] = bswap32(v3.x); w[13] = bswap32(v3.y); w[14] = bswap32(v3.z); w[15] = bswap32(v3.w);
+}
+
+__device__ __forceinline__ void store_digest(uint8_t* out, const uint32_t (&h)[8]) {
+    uint4 lo, hi;
+    lo.x = bswap32(h[0]); lo.y = bswap32(h[1]); lo.z = bswap32(h[2]); lo.w = bswap32(h[3]);
+    hi.x = bswap32(h[4]); hi.y = bswap32(h[5]); hi.z = bswap32(h[6]); hi.w = bswap32(h[7]);
+    uint4* o = reinterpret_cast<uint4*>(out);
+    o[0] = lo; o[1] = hi;
+}
+
 }  // namespace mxd

@@ -94,6 +94,7 @@ class Engine:
         self._ctx = C.c_void_p()
         self._parent = None
         devs = list(devices) if devices is not None else []
+        self._devices = devs
         arr = (C.c_int * max(len(devs), 1))(*devs)
         self._check(self._lib.mxd_open(C.byref(self._ctx), arr if devs else None, len(devs), ring_bytes), "mxd_open")
 
@@ -107,6 +108,7 @@ class Engine:
         child._lib = self._lib
         child._ctx = C.c_void_p()
         child._parent = self
+        child._devices = self._devices
         self._check(self._lib.mxd_op_begin(self._ctx, C.byref(child._ctx)), "mxd_op_begin")
         import weakref
         if not hasattr(self, "_children"):
@@ -145,6 +147,13 @@ class Engine:
 
     def device_count(self) -> int:
         return self._lib.mxd_device_count(self._ctx)
+
+    def device_index(self, ordinal: int) -> int:
+        """The `dev` argument of the dev_* calls for CUDA device `ordinal`; ValueError if the engine does not drive it."""
+        devs = self._devices or list(range(self.device_count()))
+        if ordinal not in devs:
+            raise ValueError(f"cuda:{ordinal} is not one of this engine's devices {devs}")
+        return devs.index(ordinal)
 
     def stats(self) -> dict:
         st = N.Stats()
@@ -420,6 +429,15 @@ class Engine:
 
     def dev_tree_digest(self, dev: int, d_data: int, size: int, tp: Tuple[int, int, int], d_chunks: int, d_root: int, stream: int = 0):
         self._check(self._lib.mxd_dev_tree_digest(self._ctx, dev, d_data, size, _tp(*tp), d_chunks, d_root, stream), "mxd_dev_tree_digest")
+
+    def dev_tree_digest_extents(self, dev: int, extents: Sequence[Tuple[int, int]], tp: Tuple[int, int, int], d_chunks: int,
+                                d_root: int, stream: int = 0):
+        """Tree digest of the concatenation of device spans [(ptr, nbytes), ...] (mxd_dev_tree_digest_extents);
+        d_chunks may be 0.  Asynchronous on `stream`."""
+        n = len(extents)
+        arr = (N.Span * max(n, 1))(*[N.Span(p, ln) for p, ln in extents])
+        self._check(self._lib.mxd_dev_tree_digest_extents(self._ctx, dev, arr if n else None, n, _tp(*tp), d_chunks, d_root, stream),
+                    "mxd_dev_tree_digest_extents")
 
     def dev_compare(self, dev: int, d_got: int, d_want: int, n: int, d_ok: int, stream: int = 0):
         self._check(self._lib.mxd_dev_compare(self._ctx, dev, d_got, d_want, n, d_ok, stream), "mxd_dev_compare")

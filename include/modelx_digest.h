@@ -193,6 +193,36 @@ int mxd_tree_digest_file_tee(mxd_ctx*, const char* path, const mxd_tree_params* 
  * sizes and status (per file, MXD_OK or that file's I/O error) may be NULL.  Returns MXD_OK or the first failing status. */
 int mxd_tree_digest_files(mxd_ctx*, const char* const* paths, uint64_t n, const mxd_tree_params* tp, uint8_t* roots,
                           uint64_t* sizes, int* status);
+/* Load a file straight into device memory and return the tree digest of the bytes that landed there: every byte of
+ * `path` is copied into the concatenation dst[0] || dst[1] || ... || dst[n-1], device spans on device `dev` (index into
+ * the context's device list) -- e.g. a safetensors header buffer followed by one allocation per tensor -- and the
+ * leaves are hashed from those spans, not from a staging buffer.  The file is read once, through the same pinned ring
+ * as mxd_tree_digest_file, and the results are bit-identical to mxd_tree_digest_file of the same file.  `dst` is a HOST
+ * array; the library keeps no pointer to it after the call returns.  Synchronous, like the other file forms.
+ *   - Spans may start at any byte address and have any length, including 0 (skipped).  A non-empty span must be device
+ *     memory of device `dev` (its first and last byte are checked with cudaPointerGetAttributes, which cannot tell
+ *     where one allocation ends and the next begins: a span that runs past its own allocation is the caller's error),
+ *     and no two non-empty spans may share a byte: they are written.
+ *   - Returns MXD_ERR_INVALID, writes no destination byte and reads nothing of the file when the handle or `dev` is
+ *     bad, `path` or `root` is NULL, the tree parameters are invalid, n > 0 and dst == NULL, a span with a nonzero
+ *     length has a NULL pointer, the total length overflows uint64_t, a span is not device memory of `dev`, two spans
+ *     overlap, the total length is not the file's size, or chunk_digests is given with cap_chunks below the number of
+ *     chunks.  A missing file, a directory, or a file that shrinks while loading is MXD_ERR_IO; a canceled operation
+ *     MXD_ERR_CANCELED.
+ *   - On any error the destination contents are unspecified and chunk_digests, nchunks, size and root are untouched.
+ *     When the call returns, no copy into a destination and no kernel of the call is still in flight.
+ *   - Ordering: the library orders its writes to the destinations after nothing.  No work on any other stream may touch
+ *     them during the call (e.g. a caching allocator that hands back memory a queued kernel still uses: synchronise
+ *     that stream first).
+ *   - Accounting: src_bytes_read and h2d_bytes each grow by exactly the file size (the file is read once); bytes_hashed
+ *     grows as for mxd_tree_digest_file (the file size at the leaf level, plus the levels above); every leaf launch (one
+ *     per ring slot) is seen by mxd_prof_*, and every slot is recorded by mxd_trace_* with its copies into the
+ *     destinations as its H2D span.
+ *   - Device scratch: the leaf digests (32 bytes per leaf), the chunk digests and a 24-byte table entry per non-empty
+ *     span, for the duration of the call. */
+int mxd_tree_load_file(mxd_ctx*, int dev, const char* path, const mxd_span* dst, uint64_t n, const mxd_tree_params* tp,
+                       uint8_t* chunk_digests /*may be NULL*/, uint64_t cap_chunks, uint64_t* nchunks, uint64_t* size,
+                       uint8_t root[32]);
 /* Sharded form (one process per GPU): chunk digests of a piece that starts on a chunk boundary... */
 int mxd_tree_chunks(mxd_ctx*, const void* piece /*host or device*/, uint64_t nbytes, const mxd_tree_params* tp,
                     uint8_t* chunk_digests /*max(1, ceil(nbytes/chunk))*32*/);

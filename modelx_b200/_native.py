@@ -96,6 +96,8 @@ PROTOTYPES = {
     "mxd_tree_chunks": (C.c_int, [vp, vp, C.c_uint64, C.POINTER(TreeParams), u8p]),
     "mxd_tree_digest_files": (C.c_int, [vp, C.POINTER(C.c_char_p), C.c_uint64, C.POINTER(TreeParams), u8p, u64p, C.POINTER(C.c_int)]),
     "mxd_tree_chunks_file": (C.c_int, [vp, C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(TreeParams), u8p]),
+    "mxd_tree_load_file": (C.c_int, [vp, C.c_int, C.c_char_p, C.POINTER(Span), C.c_uint64, C.POINTER(TreeParams), u8p,
+                                     C.c_uint64, u64p, u64p, u8p]),
     "mxd_tree_finish": (C.c_int, [vp, u8p, C.c_uint64, C.c_uint64, C.POINTER(TreeParams), u8p]),
     "mxd_calc_parts": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(Part)]),
     "mxd_server_part_count": (C.c_int64, [C.c_int64, C.c_int]),

@@ -7,15 +7,33 @@ gives.  ``tree_digest_safetensors`` computes the ``modelx.tree.v1`` digest of th
 ``modelx.tree.v1`` annotation of that file -- after a pull, to check a loaded model against its manifest; before a push,
 to annotate a checkpoint that is still in GPU memory.
 
+``load_safetensors`` is the pull-side counterpart: it reads a ``.safetensors`` file once, through the engine's pinned
+ring, straight into one new CUDA tensor per entry (``mxd_tree_load_file``), and returns the tree digest of the bytes
+that landed in those tensors; with ``expect`` it refuses weights that do not match the manifest.
+
 Imports torch on first use; ``modelx_b200`` itself does not import this module.
 """
 from __future__ import annotations
 
 import json
+import os
 import struct
-from typing import List, Mapping, Optional, Tuple
+from typing import List, Mapping, Optional, Tuple, Union
 
-from .engine import DEFAULT_CHUNK, DEFAULT_FANOUT, DEFAULT_LEAF, Engine
+from .engine import DEFAULT_CHUNK, DEFAULT_FANOUT, DEFAULT_LEAF, Engine, digest_parse
+
+MAX_HEADER_BYTES = 100 << 20     # a safetensors JSON header larger than this is not taken from outside input
+
+
+class DigestMismatch(ValueError):
+    """The loaded bytes do not have the expected tree root.  Carries what was computed -- ``root``, ``chunk_digests``
+    (one per chunk of the file, so the first differing chunk locates the damage) and ``size`` -- and ``expected``."""
+
+    def __init__(self, path: str, expected: bytes, root: bytes, chunk_digests: List[bytes], size: int):
+        from .engine import digest_string
+        super().__init__(f"{path}: tree root {digest_string(root)}, expected {digest_string(expected)}")
+        self.path, self.expected, self.root, self.chunk_digests, self.size = path, expected, root, chunk_digests, size
+
 
 # safetensors dtype string -> (torch dtype attribute, bytes per element)
 _DTYPES = {
@@ -161,3 +179,64 @@ def tree_digest_safetensors(engine: Engine, header: bytes, tensors: Mapping[str,
         st.synchronize()
         raw = d_out.cpu().numpy().tobytes()
     return [raw[32 * i:32 * i + 32] for i in range(nchunks)], raw[nchunks * 32:], len(header) + payload
+
+
+def _expected_root(expect: Union[bytes, str, None]) -> Optional[bytes]:
+    if expect is None:
+        return None
+    if isinstance(expect, (bytes, bytearray)):
+        if len(expect) != 32:
+            raise ValueError(f"expect: a raw root is 32 bytes, got {len(expect)}")
+        return bytes(expect)
+    if isinstance(expect, str):
+        try:
+            return digest_parse(expect)
+        except RuntimeError as e:
+            raise ValueError(f"expect: {e}") from None
+    raise ValueError(f"expect: want 32 bytes or 'sha256:<hex>', got {type(expect).__name__}")
+
+
+def load_safetensors(engine: Engine, path: str, device=None, expect: Union[bytes, str, None] = None,
+                     chunk: int = DEFAULT_CHUNK, leaf: int = DEFAULT_LEAF, fanout: int = DEFAULT_FANOUT):
+    """Load a ``.safetensors`` file into new CUDA tensors on `device` (default: the current CUDA device), reading the
+    file once through the engine's pinned ring, and tree-digest the bytes that landed in them.
+
+    Every tensor is its own allocation, as ``safetensors.torch.load_file`` returns them.  `expect` (raw 32 bytes or
+    ``"sha256:<hex>"``) is the tree root the file must have; on a mismatch ``DigestMismatch`` is raised and no tensor
+    is returned.  -> (tensors: dict in header order, chunk_digests, root, size), where root and chunk digests equal
+    ``Engine.tree_digest_file(path)``."""
+    import torch
+    want = _expected_root(expect)
+    with open(path, "rb") as f:
+        raw = f.read(8)
+        if len(raw) < 8:
+            raise ValueError(f"{path}: shorter than the 8-byte safetensors header length")
+        (n,) = struct.unpack("<Q", raw)
+        if n > MAX_HEADER_BYTES:
+            raise ValueError(f"{path}: safetensors header of {n} bytes is over the {MAX_HEADER_BYTES}-byte limit")
+        header = raw + f.read(n)
+        file_size = os.fstat(f.fileno()).st_size
+    entries, payload = parse_safetensors_header(header)
+    if len(header) + payload != file_size:
+        raise ValueError(f"{path}: header + tensors are {len(header) + payload} bytes, the file has {file_size}")
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if device.type != "cuda":
+        raise ValueError(f"device {device} is not a CUDA device")
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    dev = engine.device_index(device.index)
+    with torch.cuda.device(device):
+        d_header = torch.empty(len(header), dtype=torch.uint8, device=device)
+        tensors = {name: torch.empty(ent["shape"], dtype=getattr(torch, _DTYPES[ent["dtype"]][0]), device=device)
+                   for name, ent in entries.items()}
+        order = sorted(entries, key=lambda k: entries[k]["data_offsets"][0])
+        extents = [(d_header.data_ptr(), len(header))] + \
+            [(tensors[k].data_ptr(), tensors[k].numel() * tensors[k].element_size()) for k in order]
+        # the caching allocator may have handed out memory that work still queued on this stream is using
+        torch.cuda.current_stream(device).synchronize()
+        chunks, root, size = engine.tree_load_file(dev, path, extents, chunk, leaf, fanout)
+    del d_header
+    if want is not None and root != want:
+        tensors = None
+        raise DigestMismatch(path, want, root, chunks, size)
+    return tensors, chunks, root, size

@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import os
 from typing import Optional
 
 from . import _native as N
@@ -41,6 +42,26 @@ def untgz(archive: str, intodir: str, lib=None) -> None:
     """UnTGZ (pkg/client/helper.go:55-83)."""
     lib = lib or N.load()
     N.check(lib.mxc_untgz(archive.encode(), intodir.encode()), "mxc_untgz", lib)
+
+
+def _tree_identity(desc: dict):
+    """The modelx.tree.v1 root ("sha256:<hex>") and tree parameters of a manifest descriptor, in either form
+    client_host.cpp writes: tree-keyed (``digest`` is the root, annotation ``modelx.digest = "tree.v1;leaf=..."``) or
+    whole-file keyed with a tree annotation (``modelx.tree.v1 = "sha256:<root>;leaf=..."``)."""
+    ann = desc.get("annotations") or {}
+    if str(ann.get("modelx.digest", "")).startswith("tree.v1;"):
+        root, fields = desc.get("digest"), ann["modelx.digest"].split(";")[1:]
+    elif "modelx.tree.v1" in ann:
+        root, *fields = str(ann["modelx.tree.v1"]).split(";")
+    else:
+        raise ValueError(f"blob {desc.get('name')!r} has no modelx.tree.v1 identity, only a whole-file SHA-256, which is "
+                         "one serial chain the GPU cannot verify fast: push it with --tree")
+    kv = dict(f.split("=", 1) for f in fields if "=" in f)
+    try:
+        params = {k: int(kv[k]) for k in ("chunk", "leaf", "fanout")}
+    except (KeyError, ValueError):
+        raise ValueError(f"blob {desc.get('name')!r}: malformed tree parameters {';'.join(fields)!r}") from None
+    return root, params
 
 
 class LocalRegistry:
@@ -190,6 +211,22 @@ class Client:
                                                   registry.basepath.encode(), repository.encode(), version.encode(),
                                                   C.byref(out)), "mxc_push_local_tree")
         return self._report(_take(self._lib, out))
+
+    def load_safetensors(self, registry: LocalRegistry, repository: str, version: str, name: str, device=None) -> dict:
+        """Load the ``.safetensors`` blob `name` of a pushed version straight from the store into CUDA tensors on
+        `device`, verified against the tree root its manifest carries (checkpoint.load_safetensors): the blob is read
+        once, and no copy of it is written.  -> {tensor name: tensor}; DigestMismatch when the stored bytes are not
+        the pushed ones."""
+        from .checkpoint import load_safetensors
+        manifest = json.loads(registry.get_manifest_json(repository, version))
+        descs = [d for d in manifest.get("blobs") or [] if d.get("name") == name]
+        if not descs:
+            raise ValueError(f"{repository}:{version} has no blob named {name!r}")
+        desc = descs[0]
+        root, params = _tree_identity(desc)
+        path = os.path.join(registry.basepath, blob_digest_path(repository, desc["digest"], self._lib))
+        tensors, _, _, _ = load_safetensors(self.engine, path, device, expect=root, **params)
+        return tensors
 
     def pull(self, registry: LocalRegistry, repository: str, version: str, into: str) -> list:
         """Client.Pull (pull.go:19-39) against the in-process FS store; copies are verified while they are written."""

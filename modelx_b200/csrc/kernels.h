@@ -74,16 +74,18 @@ uint32_t leaf_fusable_levels(uint32_t fanout, uint32_t want);
 // [start, start + len) of the concatenation.
 struct DevExtent { const void* ptr; uint64_t len; uint64_t start; };
 
-// The leaf level of a tree digest over a concatenation of extents: leaf i = SHA-256 of bytes [i*leaf, min((i+1)*leaf,
-// size)) of the concatenation (one empty leaf when size == 0), written to out + 32 i.
+// The leaf level of a tree digest over a concatenation of extents, or a window of it: leaf i = SHA-256 of bytes
+// [i*leaf, min((i+1)*leaf, size)) of the concatenation (one empty leaf when size == 0).  A launch hashes leaves
+// [first, first + n0) and writes leaf first + i to out + 32 i; only those leaves' bytes are read.
 struct ExtentLeafJob {
     const DevExtent* ext;    // device table of m extents in concatenation order (may be NULL when m == 0)
     uint64_t m;
     uint64_t size;           // sum of the extent lengths
     uint64_t leaf;           // bytes per leaf, multiple of 64
-    uint64_t n0;             // max(1, ceil(size / leaf))
+    uint64_t n0;             // leaves in this launch; first + n0 <= max(1, ceil(size / leaf))
     uint8_t* out;            // n0 * 32 bytes, 16-byte aligned
     uint32_t one;
+    uint64_t first;          // index of the first leaf (0: the whole leaf level when n0 covers it)
 };
 cudaError_t launch_tree_leaves_extents(const ExtentLeafJob& job, cudaStream_t stream);
 

@@ -391,6 +391,59 @@ int stream_leaves(Core* c, const CancelScope& cs, DevState* d, const Tree& t, ui
     return MXD_OK;
 }
 
+// Stream [0, size) of `src` through device `d`'s pinned ring straight into the caller's device spans (`table`: the
+// non-empty spans with their offsets in the concatenation, `d_table` its device copy) and hash the leaves of every slot
+// from the spans with k_tree_leaves_extents, writing leaf digests to d_leaves (n0 * 32 bytes).  Slots hold whole
+// leaves.  The H2D copies of a slot go on the copy stream, its kernel on the compute stream after them; the kernel never
+// reads the pinned slot, so a slot is refilled as soon as its own copies are done.
+int load_leaves(Core* c, const CancelScope& cs, DevState* d, const Tree& t, const Source& src, uint64_t size,
+                const std::vector<mxd::DevExtent>& table, const mxd::DevExtent* d_table, uint8_t* d_leaves) {
+    const uint64_t per_slot = (d->slot_bytes / t.leaf) * t.leaf;
+    if (per_slot == 0) return fail(MXD_ERR_INVALID, "ring slot smaller than one leaf; raise ring_bytes");
+    auto leaves = [&](uint64_t first, uint64_t count, uint64_t nbytes) -> int {
+        ProfScope prof(c, nbytes, d->compute);
+        mxd::ExtentLeafJob j{};
+        j.ext = d_table; j.m = table.size(); j.size = size; j.leaf = t.leaf; j.first = first; j.n0 = count;
+        j.out = d_leaves + first * 32; j.one = 1;
+        MXD_CUDA(mxd::launch_tree_leaves_extents(j, d->compute));
+        c->launches++; c->bytes_hashed += nbytes;
+        return MXD_OK;
+    };
+    if (size == 0) return leaves(0, 1, 0);
+    size_t e = 0;                  // first span that ends after `off`
+    uint64_t off = 0;
+    for (uint64_t i = 0; off < size; ++i) {
+        if (cs.canceled()) return fail(MXD_ERR_CANCELED, "canceled");
+        const int s = (int)(i % kSlots);
+        const uint64_t n = (size - off < per_slot) ? size - off : per_slot;
+        if (i >= (uint64_t)kSlots) MXD_CUDA(cudaEventSynchronize(d->ev_copied[s]));
+        uint8_t* h_slot = d->h_ring + (uint64_t)s * d->slot_bytes;
+        const uint8_t* from = nullptr;
+        const double f0 = c->trace_on.load() ? now_ms() : 0;
+        int rc = source_stage(c, src, off, n, h_slot, &from, d->pool);
+        if (rc != MXD_OK) return rc;
+        TraceSlot tr(c, d->ordinal, s, n, c->trace_on.load() ? now_ms() - f0 : 0);
+        if (tr.on) cudaEventRecord(tr.rec.c0, d->copy);
+        for (size_t k = e; k < table.size() && table[k].start < off + n; ++k) {     // the pieces of the spans in this slot
+            const uint64_t a = std::max(table[k].start, off), b = std::min(table[k].start + table[k].len, off + n);
+            MXD_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(const_cast<void*>(table[k].ptr)) + (a - table[k].start), from + (a - off),
+                                     b - a, cudaMemcpyHostToDevice, d->copy));
+        }
+        while (e < table.size() && table[e].start + table[e].len <= off + n) ++e;
+        if (tr.on) cudaEventRecord(tr.rec.c1, d->copy);
+        MXD_CUDA(cudaEventRecord(d->ev_copied[s], d->copy));
+        MXD_CUDA(cudaStreamWaitEvent(d->compute, d->ev_copied[s], 0));
+        if (tr.on) cudaEventRecord(tr.rec.k0, d->compute);
+        rc = leaves(off / t.leaf, (n + t.leaf - 1) / t.leaf, n);
+        if (rc != MXD_OK) return rc;
+        if (tr.on) cudaEventRecord(tr.rec.k1, d->compute);
+        tr.commit();
+        c->h2d += n;
+        off += n;
+    }
+    return MXD_OK;
+}
+
 // chunk digests of a host/file piece on one device; result left in device memory d_chunks
 int stream_tree_chunks(Core* c, const CancelScope& cs, DevState* d, const Tree& t, const Source& src, uint64_t nbytes, uint8_t* d_chunks) {
     const uint64_t n0 = nbytes ? (nbytes + t.leaf - 1) / t.leaf : 1;
@@ -549,13 +602,15 @@ namespace mxd {
 // mxd_dev_tree_digest_extents runs unchanged.  The CUDA build never compiles this.
 cudaError_t launch_tree_leaves_extents(const ExtentLeafJob& j, cudaStream_t st) {
     if (j.n0 == 0 || (j.size != 0 && (j.m == 0 || j.ext == nullptr)) || j.out == nullptr) return cudaErrorInvalidValue;
+    if (j.first != 0 && j.first * j.leaf >= j.size) return cudaErrorInvalidValue;
     uint8_t* cat = nullptr;
     cudaError_t e = cudaMallocAsync(&cat, j.size ? j.size : 1, st);
     for (uint64_t i = 0; e == cudaSuccess && i < j.m; ++i)
         e = cudaMemcpyAsync(cat + j.ext[i].start, j.ext[i].ptr, j.ext[i].len, cudaMemcpyDeviceToDevice, st);
     if (e == cudaSuccess) {
+        const uint64_t skip = j.first * j.leaf;     // leaves [first, first + n0): the segments from byte first * leaf on
         MsgJob m{};
-        m.base = cat; m.nbytes = j.size; m.seg = j.leaf; m.nmsg = j.n0; m.out = j.out; m.finalize = 1; m.one = j.one;
+        m.base = cat + skip; m.nbytes = j.size - skip; m.seg = j.leaf; m.nmsg = j.n0; m.out = j.out; m.finalize = 1; m.one = j.one;
         e = launch_sha256(m, st);
     }
     if (cat) cudaFreeAsync(cat, st);
@@ -1085,6 +1140,95 @@ int mxd_tree_digest_file_tee(mxd_ctx* h, const char* path, const mxd_tree_params
     close(fd);
     if (rc != MXD_OK) return rc;
     return host_tree_finish(h->core, h->core->devs[0], t, chunks, nchunks, size, root);
+}
+
+int mxd_tree_load_file(mxd_ctx* h, int dev, const char* path, const mxd_span* dst, uint64_t n, const mxd_tree_params* tp,
+                       uint8_t* chunk_digests, uint64_t cap_chunks, uint64_t* nchunks_out, uint64_t* size_out, uint8_t root[32]) {
+    Tree t;
+    if (!DEV_ARGS_OK(h, dev) || !path || !root || !tree_resolve(tp, &t) || (n && !dst))
+        return fail(MXD_ERR_INVALID, "tree_load_file: bad arguments");
+    Core* c = h->core;
+    DevState* d = c->devs[dev];
+    // the destination table: non-empty spans in order, each with its offset in the concatenation
+    std::vector<mxd::DevExtent> table;
+    uint64_t total = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uintptr_t p = reinterpret_cast<uintptr_t>(dst[i].ptr);
+        const uint64_t len = dst[i].len;
+        if (len == 0) continue;
+        const std::string which = "tree_load_file: destination " + std::to_string(i);
+        if (!p) return fail(MXD_ERR_INVALID, which + " is NULL with a nonzero length");
+        if (len > ~0ull - total) return fail(MXD_ERR_INVALID, "tree_load_file: total length overflows 64 bits");
+        if (len - 1 > UINTPTR_MAX - p) return fail(MXD_ERR_INVALID, which + " runs past the end of the address space");
+        int first_ord = -1, last_ord = -1;
+        if (classify(dst[i].ptr, &first_ord) != MemKind::Device || first_ord != d->ordinal ||
+            classify(reinterpret_cast<const void*>(p + len - 1), &last_ord) != MemKind::Device || last_ord != d->ordinal)
+            return fail(MXD_ERR_INVALID, which + " is not device memory of device " + std::to_string(d->ordinal));
+        table.push_back({dst[i].ptr, len, total});
+        total += len;
+    }
+    // the spans are written, so no two may share a byte
+    std::vector<const mxd::DevExtent*> by_addr;
+    for (const auto& x : table) by_addr.push_back(&x);
+    std::sort(by_addr.begin(), by_addr.end(), [](const mxd::DevExtent* a, const mxd::DevExtent* b) { return a->ptr < b->ptr; });
+    for (size_t i = 1; i < by_addr.size(); ++i)
+        if (static_cast<const uint8_t*>(by_addr[i - 1]->ptr) + by_addr[i - 1]->len > static_cast<const uint8_t*>(by_addr[i]->ptr))
+            return fail(MXD_ERR_INVALID, "tree_load_file: destinations overlap");
+    const CancelScope cs(h);
+    if (cs.canceled()) return fail(MXD_ERR_CANCELED, "canceled");
+    int fd = open(path, O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return fail(MXD_ERR_IO, std::string("open ") + path + ": " + strerror(errno));
+    struct stat st;
+    if (fstat(fd, &st) != 0) { int e = errno; close(fd); return fail(MXD_ERR_IO, std::string("fstat: ") + strerror(e)); }
+    if (S_ISDIR(st.st_mode)) { close(fd); return fail(MXD_ERR_IO, std::string("read ") + path + ": is a directory"); }
+    const uint64_t size = (uint64_t)st.st_size;
+    if (size != total) {
+        close(fd);
+        return fail(MXD_ERR_INVALID, "tree_load_file: destinations hold " + std::to_string(total) + " bytes, the file has " + std::to_string(size));
+    }
+    const uint64_t nchunks = size ? (size + t.chunk - 1) / t.chunk : 1;
+    if (chunk_digests && cap_chunks < nchunks) { close(fd); return fail(MXD_ERR_INVALID, "tree_load_file: chunk_digests too small"); }
+    const uint64_t n0 = size ? (size + t.leaf - 1) / t.leaf : 1;
+
+    std::lock_guard<std::mutex> lk(d->mu);
+    DeviceGuard guard(d->ordinal);
+    Source src; src.fd = fd;
+    FileMapGuard fm; fm.attach(&src, size);             // unmapped after the final synchronisation
+    cudaStream_t cst = d->compute;
+    mxd::DevExtent* d_table = nullptr;
+    uint8_t *ws = nullptr, *d_out = nullptr;            // leaf digests; [chunk digests][root]
+    std::vector<uint8_t> h_out(nchunks * 32 + 32);
+    cudaError_t e = cudaMallocAsync(&ws, n0 * 32, cst);
+    if (e == cudaSuccess) e = cudaMallocAsync(&d_out, nchunks * 32 + 32, cst);
+    if (e == cudaSuccess && !table.empty()) {
+        e = cudaMallocAsync(&d_table, table.size() * sizeof(mxd::DevExtent), cst);
+        // from pageable memory: returns once `table` has been staged
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(mxd::DevExtent), cudaMemcpyHostToDevice, cst);
+    }
+    int rc = (e == cudaSuccess) ? MXD_OK : fail(MXD_ERR_CUDA, std::string("tree_load_file: ") + cudaGetErrorString(e));
+    if (rc == MXD_OK) rc = load_leaves(c, cs, d, t, src, size, table, d_table, ws);
+    if (rc == MXD_OK) rc = enqueue_levels_to_chunks(c, t, 0, ws, n0, d_out, cst);
+    if (rc == MXD_OK) rc = enqueue_tree_finish(c, t, d_out, nchunks, size, d_out + nchunks * 32, cst);
+    if (rc == MXD_OK) {
+        e = cudaMemcpyAsync(h_out.data(), d_out, nchunks * 32 + 32, cudaMemcpyDeviceToHost, cst);
+        if (e != cudaSuccess) rc = fail(MXD_ERR_CUDA, std::string("tree_load_file: ") + cudaGetErrorString(e));
+    }
+    // nothing may still be writing the destinations or reading the file mapping when the call returns
+    const cudaError_t e_copy = cudaStreamSynchronize(d->copy);
+    const cudaError_t e_comp = cudaStreamSynchronize(cst);
+    if (rc == MXD_OK && (e_copy != cudaSuccess || e_comp != cudaSuccess))
+        rc = fail(MXD_ERR_CUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e_copy != cudaSuccess ? e_copy : e_comp));
+    if (d_table) cudaFreeAsync(d_table, cst);
+    if (ws) cudaFreeAsync(ws, cst);
+    if (d_out) cudaFreeAsync(d_out, cst);
+    close(fd);
+    if (rc != MXD_OK) return rc;
+    c->d2h += nchunks * 32 + 32;
+    if (chunk_digests) memcpy(chunk_digests, h_out.data(), nchunks * 32);
+    memcpy(root, h_out.data() + nchunks * 32, 32);
+    if (nchunks_out) *nchunks_out = nchunks;
+    if (size_out) *size_out = size;
+    return MXD_OK;
 }
 
 int mxd_tree_chunks_file(mxd_ctx* h, const char* path, uint64_t offset, uint64_t nbytes, const mxd_tree_params* tp, uint8_t* out) {

@@ -2,8 +2,9 @@
 // in HBM is a header plus a few hundred tensor allocations, and its tree digest is that of their concatenation.
 //
 // One lane per leaf, 64-thread CTAs, 12 CTAs per SM (the same 80-register budget as k_sha256_lanes).  Leaf i is the
-// logical range [i*leaf, min((i+1)*leaf, size)) of the concatenation.  A lane binary-searches the extent table for the
-// extent holding its first byte and then walks forward through the table.
+// logical range [i*leaf, min((i+1)*leaf, size)) of the concatenation; lane i of a launch hashes leaf first + i, so a
+// streaming caller (mxd_tree_load_file) can hash one ring slot's leaves at a time against the whole table.  A lane
+// binary-searches the extent table for the extent holding its first byte and then walks forward through the table.
 //
 // Fast loop: while every lane of a group has its next blocks wholly inside one extent and all of them share the same
 // address class a = addr & 15, the group runs a straight-line loop specialised on a (the warp-minimum number of blocks
@@ -111,10 +112,10 @@ __device__ __forceinline__ void gather_block(Cursor& c, const DevExtent* ext, co
 }
 
 __global__ void __launch_bounds__(kThreads, 12) k_tree_leaves_extents(const ExtentLeafJob j) {
-    const uint64_t leaf_idx = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
+    const uint64_t lane = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
     const uint32_t one = j.one;
-    const bool live = leaf_idx < j.n0;
-    const uint64_t lo = leaf_idx * j.leaf;
+    const bool live = lane < j.n0;
+    const uint64_t lo = (j.first + lane) * j.leaf;
     const uint64_t len = (live && lo < j.size) ? ((j.size - lo < j.leaf) ? j.size - lo : j.leaf) : 0;
     const uint64_t nfull = len >> 6;
     const uint32_t r = (uint32_t)(len & 63u);
@@ -164,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, 12) k_tree_leaves_extents(const Exte
             ++b;
         }
     }
-    if (live) store_digest(j.out + 32 * leaf_idx, h);
+    if (live) store_digest(j.out + 32 * lane, h);
 }
 
 }  // namespace

@@ -371,6 +371,27 @@ class Engine:
         raw = bytes(chunks)
         return [raw[32 * i:32 * i + 32] for i in range(got.value)], bytes(root), sz.value
 
+    def tree_load_file(self, dev: int, path: str, extents: Sequence[Tuple[int, int]], chunk: int = DEFAULT_CHUNK,
+                       leaf: int = DEFAULT_LEAF, fanout: int = DEFAULT_FANOUT):
+        """Copy the file into the device spans [(ptr, nbytes), ...] on device index `dev`, whose lengths must add up to
+        the file size, and tree-digest the bytes that landed there (mxd_tree_load_file).  Synchronous; nothing else
+        may touch the spans during the call.  -> (chunk_digests, root, size), as ``tree_digest_file`` of the file."""
+        import os
+        try:
+            size = os.stat(path).st_size
+        except OSError:
+            size = 0                  # the call reports the missing file
+        n = len(extents)
+        arr = (N.Span * max(n, 1))(*[N.Span(p, ln) for p, ln in extents])
+        nch = max(1, -(-size // chunk))
+        chunks = (C.c_uint8 * (32 * nch))()
+        got, sz = C.c_uint64(), C.c_uint64()
+        root = (C.c_uint8 * 32)()
+        self._check(self._lib.mxd_tree_load_file(self._ctx, dev, path.encode(), arr if n else None, n, _tp(chunk, leaf, fanout),
+                                                 chunks, nch, C.byref(got), C.byref(sz), root), "mxd_tree_load_file")
+        raw = bytes(chunks)
+        return [raw[32 * i:32 * i + 32] for i in range(got.value)], bytes(root), sz.value
+
     def tree_chunks_ptr(self, ptr: int, n: int, chunk: int = DEFAULT_CHUNK, leaf: int = DEFAULT_LEAF,
                         fanout: int = DEFAULT_FANOUT) -> bytes:
         nch = max(1, -(-n // chunk))
